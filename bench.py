@@ -19,11 +19,16 @@ same public API with the batch copied from pinned host memory and the loss read 
 ``--overlap`` (one rank per GPU only) captures the step as ONE CUDA graph of forward, backward and
 ``sync_model`` with backward overlap enabled (``distrib.overlap(model)``: gradient buckets leave on
 the communicator's side stream while backward still runs; ``sync_model`` sends the tail bucket and
-joins).  It is off by default: on this latency-bound batch-64 step it measured slower than one exposed
-``sync_model`` launch (profiles/README.md).  Before anything is timed, at every N, the real 62-tensor bf16 gradient
-bucket is averaged once with seeded inputs and compared with ``oracle/numeric.py`` (checker use
-only, outside every timed region): the ``parity`` object, and a non-zero exit on mismatch.
-``--model resnet50 --image 224 --batch 32`` is BASELINE configs[2].
+joins).  It is off by default: every bucket kernel brings a fixed latency and takes whole SMs from
+backward, and on an earlier target (B200) the batch-64 step measured slower with it; not yet re-measured
+on H100, where it needs one rank per GPU.  Before anything is timed, at every N,
+the real 62-tensor bf16 gradient bucket is averaged once with seeded inputs and compared with
+``oracle/numeric.py`` (checker use only, outside every timed region): the ``parity`` object, and a
+non-zero exit on mismatch.  ``--model resnet50 --image 224 --batch 32`` is BASELINE configs[2].
+
+``--dump-outputs DIR`` writes, after the K timed steps, what the last of them handed its caller, as
+float32 ``.npy`` files (see ``dump_outputs``).  Every input is seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -59,9 +64,12 @@ def parse():
     ap.add_argument("--model", default="resnet18", choices=("resnet18", "resnet50"))
     ap.add_argument("--image", type=int, default=32, help="square image size (32: CIFAR, 224: ImageNet-shaped)")
     ap.add_argument("--overlap", action="store_true",
-                    help="capture the step with distrib.overlap(model): gradient buckets leave during backward (measured slower "
-                         "for this latency-bound step, see profiles/README.md; default: one sync_model launch after backward)")
+                    help="capture the step with distrib.overlap(model): gradient buckets leave during backward (default: one "
+                         "sync_model launch after backward)")
     ap.add_argument("--no-parity", action="store_true", help="skip the pre-timing parity check against the oracle")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the last step's loss, averaged gradients and updated parameters "
+                         "of this process's ranks to DIR/*.npy (float32; a fixed seeded sample of the gradients and parameters)")
     return ap.parse_args()
 
 
@@ -231,15 +239,49 @@ class Replica:
         if self.graph is not None:
             self.graph.replay()
         else:
+            self.optim.zero_grad()                                    # at the start: .grad keeps the step's result
             self.loss.copy_(self._fwd_bwd().detach())
         if not (self.overlap and self.graph is not None):
             self.distrib.sync_model(self.model)
         self.optim.step()
-        if self.graph is None:
-            self.optim.zero_grad()
         if e2e:
             return self.loss.item()                                   # device -> host read of the step's result
         return None
+
+
+DUMP_SAMPLE = 1 << 19         # flat gradient / parameter indices stored per rank by --dump-outputs
+
+
+def dump_outputs(out_dir: str, replicas) -> None:
+    """What the last timed step handed its caller, for every rank this process hosts (all of them with
+    ``--gpus 1``), in rank order:
+        loss.npy          [ranks]      the step's loss
+        grad_sample.npy   [ranks, S]   the gradients ``sync_model`` averaged (left in ``.grad``)
+        param_sample.npy  [ranks, S]   the parameters after ``optim.step()``
+        sample_index.npy  [S]          flat indices (float64) into the concatenated parameter list
+    The model does not fit the 64 MB budget of a dump, so gradients and parameters are sampled at
+    S = DUMP_SAMPLE indices drawn once from a fixed seed: the same indices in every run."""
+    import numpy as np
+    import torch
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    torch.cuda.synchronize()
+    total = sum(p.numel() for p in replicas[0].model.parameters())
+    idx = np.sort(np.random.default_rng(0).choice(total, size=min(DUMP_SAMPLE, total), replace=False))
+    pick = torch.from_numpy(idx)
+
+    def sample(tensors):
+        return torch.cat([t.detach().reshape(-1).float().cpu() for t in tensors])[pick].numpy()
+    grads, params = [], []
+    for rep in replicas:
+        ps = list(rep.model.parameters())
+        assert all(p.grad is not None for p in ps), "a parameter has no gradient after the timed step"
+        grads.append(sample([p.grad for p in ps]))
+        params.append(sample(ps))
+    np.save(out / "loss.npy", np.array([float(rep.loss) for rep in replicas], dtype=np.float32))
+    np.save(out / "grad_sample.npy", np.stack(grads).astype(np.float32))
+    np.save(out / "param_sample.npy", np.stack(params).astype(np.float32))
+    np.save(out / "sample_index.npy", idx.astype(np.float64))
 
 
 def bf16_ulp_distance(a, b) -> int:
@@ -384,21 +426,15 @@ def native_arm(args) -> None:
     if cuprof:
         torch.cuda.synchronize()
         torch.cuda.profiler.stop()
+    if args.dump_outputs and proc_rank == 0:
+        dump_outputs(args.dump_outputs, replicas)                    # before any further step changes them
     # kernels of this library inside the timed region: host-side launches plus the ones each graph replay re-issues
     launches = eng.native_launches() - launches0 + args.steps * sum(rep.launches_per_replay for rep in replicas)
     # ---- timed: K steps end to end (H2D batch + D2H loss inside the region)
     ms_e2e = timed_region(args.steps, e2e=True)
-    # The timed regions are short (tens of ms at 8 GPUs): keep the same load running until the
-    # sampler has had ~0.6 s, so that the median SM clock under load rests on enough samples.
-    # Collective: every rank runs the same number of extra (untimed) steps.
-    t_load = ms_value + ms_e2e
-    extra = 0
-    while t_load < 600.0 and extra < 40:
-        t_load += timed_region(args.steps, e2e=False)
-        extra += 1
     clocks = sampler.stop() if sampler else None
     if clocks is not None:
-        clocks["sampled_over_ms"] = t_load
+        clocks["sampled_over_ms"] = ms_value + ms_e2e
 
     # ---- the dominant kernel of this repo, timed live: the whole gradient+buffer bucket of one sync_model call as
     # ONE launch (backward overlap switched off), CUDA events around every launch on its launch stream
@@ -463,29 +499,18 @@ def native_arm(args) -> None:
         info = eng.plans[grad_key].info
         kernel = N.KERNEL_NAMES.get(int(info.kernel), "?")
         payload = sum(grad_key[1]) * 2                                # bf16 bytes of one rank's bucket (N)
-        peaks = {}
-        try:
-            peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
-        except OSError:
-            pass
         if n_local == W:
             # all ranks on this GPU: every byte moves through HBM.  Per rank: pack 2N, reduce reads N
             # and writes N/W, gather reads N and writes N  ->  (5 + 1/W) N, times the W hosted ranks.
             alg_bytes = W * (5 + 1 / W) * payload
-            peak, bound, peak_src = peaks.get("hbm_gbs", 6650.0), "hbm", ("measured" if peaks else "fallback")
+            peak, bound, peak_src = 3350.0, "hbm", "H100 SXM data sheet: HBM3 3.35 TB/s"
         else:
             # NVLink bytes per GPU per direction in the all-reduce bus-bandwidth convention
             # (reduce-scatter + all-gather of the shards held elsewhere): 2 n_local (W - n_local) / W * N
             alg_bytes = 2 * n_local * (W - n_local) / W * payload
-            peak, bound, peak_src = 900.0, "nvlink", "nominal NVLink 5 per direction (measured peer copy: 770)"
+            peak, bound, peak_src = 450.0, "nvlink", "H100 SXM data sheet: NVLink 4, 900 GB/s bidirectional = 450 per direction"
         achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9
-        traffic = None
-        try:
-            traffic = json.loads((ROOT / "profiles" / "traffic.json").read_text()).get(f"{kernel}@n{n_gpus}")
-        except (OSError, ValueError):
-            pass
         roofline = {"bound": bound, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "traffic": traffic,
                     "kernel": f"{kernel} ({N.ALGO_NAMES.get(int(info.algo), '?')}, grid {int(info.grid_x)} x {n_local}, "
                               f"{int(info.chunks)} chunks of {int(info.chunk_bytes)} B per slice): the gradient+buffer bucket of one "
                               f"sync_model call, {len(grad_key[1])} tensors",
@@ -515,7 +540,8 @@ def native_arm(args) -> None:
                                 ".grad (same state as zero_grad(set_to_none=True) + backward)" if not args.no_graphs
                                 else "optim.zero_grad() every step"),
                   "l2": "not flushed: a step touches weights+grads+activations of every hosted replica; the stand-alone "
-                        "kernel timing re-reads a bucket that fits the 126 MB L2, as it does right after backward"},
+                        "kernel timing re-reads the hosted ranks' buckets back to back, which the 50 MB L2 of an H100 holds "
+                        "in part, as it does right after backward"},
         "e2e": {"value": samples / (ms_e2e * 1e-3), "unit": "samples/s", "ms_per_step": ms_e2e / args.steps,
                 "h2d_bytes_per_step": replicas[0].h2d_bytes * args.world,
                 "d2h_bytes_per_step": replicas[0].d2h_bytes * args.world,

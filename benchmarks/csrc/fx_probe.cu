@@ -1,4 +1,4 @@
-// Micro-benchmarks of the raw NVLink-5 / NVSwitch primitives the collective kernels are built
+// Micro-benchmarks of the raw NVLink / NVSwitch primitives the collective kernels are built
 // from (BENCHMARK INFRASTRUCTURE, not on the product path): multimem.ld_reduce / multimem.st
 // rates as a function of grid, block and unroll, the peer-to-peer pull rate, the same with
 // concurrent local HBM copy traffic (register copies or a cp.async.bulk ring), unloaded

@@ -10,7 +10,7 @@
 # script each rank runs is benchmarks/trace_fuse.py (a few sync_model calls on ResNet-sized gradient lists).
 # Writes OUT_PREFIX.csv (ncu raw page) and OUT_PREFIX.log.
 set -u
-N=${1:-8}; OUT=${2:-gpurun_out/ncu_rank0}; shift 2 || true
+N=${1:-8}; OUT=${2:-$(mktemp -d)/ncu_rank0}; shift 2 || true
 PORT=${MASTER_PORT:-29533}
 METRICS="gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum,launch__registers_per_thread,launch__grid_size,launch__block_size,smsp__warps_active.avg.per_cycle_active,lts__t_sectors_srcunit_tex_op_read.sum,lts__t_sectors_srcunit_tex_op_write.sum"
 export MASTER_ADDR=127.0.0.1 MASTER_PORT=$PORT WORLD_SIZE=$N FLASHY_B200_DEVICE_TIMEOUT=${FLASHY_B200_DEVICE_TIMEOUT:-20}

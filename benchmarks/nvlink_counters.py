@@ -9,7 +9,7 @@ KiB granularity) before and after ``launches`` back-to-back ``sync_model`` calls
 lists, and the kernel time comes from CUDA events around every launch.  Reported per case: NVLink bytes per
 launch and direction as counted by the hardware, next to the algorithmic figure of the algorithm in use
 ((1 + 1/W) N for the in-switch reduction, 2 (W-1)/W N peer to peer), and the resulting GB/s per direction
-against the 900 GB/s nominal / 770 GB/s measured peer-copy peak.  One JSON line per case (rank 0 prints the
+against the 450 GB/s per direction of NVLink 4 (H100 SXM data sheet).  One JSON line per case (rank 0 prints the
 max over ranks of the time and the mean over ranks of the bytes).  Benchmark infrastructure only.
 """
 from __future__ import annotations
@@ -112,7 +112,7 @@ def main():
                 rx = float(stats[2]) / world / args.launches
                 row.update(counted_tx_bytes_per_launch=tx, counted_rx_bytes_per_launch=rx,
                            counted_tx_gbs=tx / t / 1e9, counted_rx_gbs=rx / t / 1e9,
-                           frac_of_900=max(tx, rx) / t / 1e9 / 900.0, frac_of_770_measured_peer_copy=max(tx, rx) / t / 1e9 / 770.0)
+                           frac_of_450_nominal=max(tx, rx) / t / 1e9 / 450.0)
             print(json.dumps(row), flush=True)
         del model
     torch.cuda.synchronize()

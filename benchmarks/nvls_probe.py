@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Raw NVLink-5 / NVSwitch primitive rates on this box (benchmark infrastructure).
+"""Raw NVLink / NVSwitch, multimem and local-copy primitive rates of the GPUs at hand (benchmark infrastructure).
 
     torchrun --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 benchmarks/nvls_probe.py [--quick]
+    python benchmarks/nvls_probe.py --quick          # one GPU: the local copy and latency cases only
 
 Times the building blocks of the bucketed all-reduce in isolation, over the communicator's own
 arenas and multicast mapping (``fx_comm_get_pointers``): multimem.ld_reduce + multimem.st loops
@@ -111,6 +112,7 @@ def main():
 
     emit(kind="info", world=world, multicast=have_mc, mc_error=eng.multicast_error, payload_mb=args.mb,
          sm_count=int(eng.info.sm_count))
+    sms = int(eng.info.sm_count)                                     # one CTA per SM (132 on an H100 SXM)
 
     # ------------------------------------------------------------------ sanity: results of one launch
     if have_mc:
@@ -119,7 +121,7 @@ def main():
         torch.cuda.synchronize()
         dist.barrier()
         a = mkargs(pattern=1)
-        assert probe.fxp_mm(0, 148, 512, 4, C.byref(a), C.c_void_p(stream.cuda_stream)) == 0
+        assert probe.fxp_mm(0, sms, 512, 4, C.byref(a), C.c_void_p(stream.cuda_stream)) == 0
         torch.cuda.synchronize()
         dist.barrier()
         memcpy(x.data_ptr(), arenas[rank] + region, nbytes)
@@ -131,12 +133,12 @@ def main():
         dist.barrier()
     # TMA ring copy correctness
     a = mkargs(reduce_threads=0)
-    rc = probe.fxp_mix_tma(148, 32, 4, C.byref(a), C.c_void_p(stream.cuda_stream))
+    rc = probe.fxp_mix_tma(sms, 32, 4, C.byref(a), C.c_void_p(stream.cuda_stream))
     torch.cuda.synchronize()
     emit(kind="sanity", what="cp.async.bulk ring copy", rc=rc, ok=bool(torch.equal(copy_src, copy_dst)))
     copy_dst.zero_()
     a = mkargs()
-    rc = probe.fxp_mm(5, 148, 512, 8, C.byref(mkargs(pattern=1, shard_vec=2 * nbytes // 16, rank=0)), C.c_void_p(stream.cuda_stream))
+    rc = probe.fxp_mm(5, sms, 512, 8, C.byref(mkargs(pattern=1, shard_vec=2 * nbytes // 16, rank=0)), C.c_void_p(stream.cuda_stream))
     torch.cuda.synchronize()
     emit(kind="sanity", what="register copy", rc=rc, ok=bool(torch.equal(copy_src, copy_dst)))
 
@@ -158,7 +160,7 @@ def main():
         records.append((descr, e0.elapsed_time(e1) / args.launches))
 
     sptr = C.c_void_p(stream.cuda_stream)
-    grids = [16, 32, 64, 148, 296] if not args.quick else [32, 148]
+    grids = [16, 32, 64, sms, 2 * sms] if not args.quick else [32, sms]
     threads_l = [64, 128, 256, 512, 1024] if not args.quick else [512]
     unrolls = [1, 2, 4, 8, 16] if not args.quick else [4, 8]
     mode_names = {0: "ld_reduce+mc_st", 1: "ld_reduce+local_st", 2: "mc_st", 3: "p2p_pull", 4: "ld_reduce+mc_st(swp)",
@@ -177,17 +179,17 @@ def main():
                         timed(dict(kind="mm", mode=mode_names[mode], grid=grid, threads=threads, unroll=u, pattern=pattern),
                               lambda: probe.fxp_mm(mode, grid, threads, u, C.byref(a), sptr))
     # local copy alone: register copy and TMA ring (2N bytes = the pack + unpack traffic of one call)
-    for grid in (148, 296):
+    for grid in (sms, 2 * sms):
         for threads in (128, 256, 512):
             a = mkargs(pattern=1, shard_vec=2 * nbytes // 16, rank=0)
             timed(dict(kind="copy", how="registers", grid=grid, threads=threads, unroll=8),
                   lambda: probe.fxp_mm(5, grid, threads, 8, C.byref(a), sptr))
-    for grid in (148, 296):
+    for grid in (sms, 2 * sms):
         a = mkargs(reduce_threads=0)
         timed(dict(kind="copy", how="tma_ring", grid=grid, threads=32), lambda: probe.fxp_mix_tma(grid, 32, 4, C.byref(a), sptr))
     if have_mc:
         # reduce role + copy role in one CTA
-        for grid in (148, 296):
+        for grid in (sms, 2 * sms):
             for tr, tc in ((64, 256), (128, 256), (256, 256), (384, 128), (512, 256), (512, 512), (768, 256)):
                 for u in (1, 2, 4, 8):
                     a = mkargs(pattern=1, reduce_threads=tr)

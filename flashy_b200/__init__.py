@@ -1,7 +1,7 @@
-"""flashy_b200 -- a Blackwell-native implementation of ``flashy.distrib``.
+"""flashy_b200 -- a Hopper-native (H100) implementation of ``flashy.distrib``.
 
 ``flashy_b200.distrib`` exports exactly the reference module's names
-(``/root/reference/flashy/distrib.py``); see INTEGRATION.md for dropping it into a Flashy
+(the reference's ``flashy/distrib.py``); see INTEGRATION.md for dropping it into a Flashy
 checkout.  ``VirtualWorld`` hosts several virtual ranks on one GPU for rehearsal / testing.
 """
 __version__ = "0.1.0"

@@ -58,7 +58,7 @@ __device__ __forceinline__ bool block_barrier(const FxLaunch& a, int rank, int w
         const uint32_t* mine = &pad_of(a.arena[rank])->flags[b][q];
         unsigned long long t0 = 0;
         uint32_t spins = 0;
-        // (polling relaxed + one fence.acq_rel.sys afterwards measured ~5 us slower per barrier)
+        // (polling relaxed + one fence.acq_rel.sys afterwards measured slower per barrier on B200)
         while ((int32_t)(ld_acquire_sys(mine) - target) < 0) {
             if ((++spins & 0x3ff) == 0) {
                 const unsigned long long now = globaltimer_ns();
@@ -106,8 +106,8 @@ template <int OP, typename A> __device__ __forceinline__ A combine(A x, A y) {
 
 // ============================================================================ bucket <-> tensors
 // Per-CTA view of the bucket metadata.  Walking it from global memory costs a chain of
-// dependent ~1 us DRAM round trips per slice (binary search over the offsets, then the
-// pointers): measured as ~40 us of fixed latency per launch at W = 8.  So each CTA first copies
+// dependent DRAM round trips per slice (binary search over the offsets, then the
+// pointers), a large fixed latency per launch.  So each CTA first copies
 // the tables into shared memory with one coalesced pass (buckets of up to FX_SMEM_TENSORS
 // tensors; larger ones keep reading global memory).
 #define FX_SMEM_TENSORS 1024

@@ -21,9 +21,10 @@
 //   unpack  (1 warp)  arena (own after NVLS, peers' otherwise) -> shared memory -> output tensors
 //
 // Four reduce warps x U vectors per lane (U = 1 at 8 GPUs) keep 2 KiB of multimem requests in flight per
-// SM: already the measured plateau (837 of 841 GB/s bus; 64 KiB per SM drops to 770 and only adds
-// queueing in front of the flags -- profiles/r02_nvls_probe_n8.jsonl).  The reduce warps never execute
-// a system-scope fence (1.76 us unloaded, 12-18 us while the SM streams multicast stores) and never wait
+// SM: on an earlier target (B200) a few KiB per SM saturated the switch and much deeper queues only added
+// queueing in front of the flags; benchmarks/nvls_probe.py measures both, not yet on H100.  The reduce warps
+// never execute a system-scope fence (an order of magnitude dearer than a GPU-scope one on that target, more
+// so while the SM streams multicast stores) and never wait
 // for their own stores: the NVLink stream of a CTA only stalls when a peer is late.  Pieces whose tensor
 // address is not 16-byte aligned and the (< 16 byte) tails of odd-sized tensors go through ordinary
 // loads / stores of the same warp.
@@ -58,7 +59,8 @@ __device__ __forceinline__ void fence_gpu() { asm volatile("fence.acq_rel.gpu;" 
 // "chunks < n of my copy are packed": the packed data sits in THIS GPU's memory (written by bulk
 // stores that have completed), and every reader -- the switch for multimem.ld_reduce, a peer's
 // plain load -- is served by this GPU's L2, so ordering the flag behind the data at GPU scope is
-// enough; a system-scope fence costs 1.76 us here against 0.14 us (benchmarks/nvls_probe.py).
+// enough, and a GPU-scope fence was far cheaper than a system-scope one (benchmarks/nvls_probe.py, measured
+// on an earlier target, B200; not yet on H100).
 __device__ __forceinline__ void signal_packed(const FxLaunch& a, int lane, int world, int rank, int b, uint32_t value) {
     fence_gpu();
     if (lane < world) st_relaxed_sys(pipe_flag(a.arena[lane], FX_FLAG_PACK, b, rank), value);
@@ -245,8 +247,7 @@ __global__ void __launch_bounds__(FZ_THREADS, 1) k_fuse(const FxLaunch a) {
             next = covered;
             // order the flag behind the reduce warps' stores (cumulative): they went to every peer's arena with
             // NVLS (system scope), to this GPU's own arena otherwise (GPU scope is enough, see signal_packed)
-            // (holding the reduce warps' stores back for the moment of the fence was tried: fences stay 3-6 us at two
-            //  GPUs either way and the kernel gets 7-9 % slower -- profiles/r02_raw/sync_n2_pause.jsonl)
+            // (holding the reduce warps' stores back for the moment of the fence was tried on B200: it made the kernel slower)
             if (NVLS) fence_sys(); else fence_gpu();
             if (trace && lane == 0) trace[FZ_TR_SIG + 2 * (next - 1) + 1] = globaltimer_ns();
             if (lane < world) st_relaxed_sys(pipe_flag(a.arena[lane], FX_FLAG_RED, b, rank), base + (uint32_t)next);

@@ -883,8 +883,9 @@ extern "C" int fx_plan_create(fx_comm* c, int world, const int64_t* numels, int 
     const size_t data_bytes = (size_t)cur * wsize;
     const size_t one_shot_max = (size_t)env_ll("FLASHY_B200_ONE_SHOT_MAX", 256 << 10);
     const size_t nvls_min = (size_t)env_ll("FLASHY_B200_NVLS_MIN", 512 << 10);
-    // NVLS moves (1 + 1/W) N bytes per direction, the peer-to-peer two-shot 2 (W-1)/W N: the switch
-    // only wins from W = 4 up (W = 2: 1.5 N against N -- measured 276 vs 410 GB/s bus at 1 GiB).
+    // NVLS moves (1 + 1/W) N bytes per direction, the peer-to-peer two-shot 2 (W-1)/W N: at W = 2 the switch
+    // moves 1.5 N against N.  The W = 4 default of FLASHY_B200_NVLS_MIN_WORLD and the size thresholds above
+    // were tuned on an earlier target (B200, NVLink 5) and are not yet re-measured on H100.
     const bool nvls_ok = c && c->multicast && (wire_dtype == FX_F32 || wire_dtype == FX_BF16 || wire_dtype == FX_F16);
     const bool nvls_auto = nvls_ok && world >= (int)env_ll("FLASHY_B200_NVLS_MIN_WORLD", 4);
     if (algo == FX_ALGO_NVLS && !nvls_ok) { delete p; return fx_fail(FX_ERR_UNSUPPORTED, "NVLS handles fp32 / bf16 / fp16 buckets only"); }
@@ -898,7 +899,7 @@ extern "C" int fx_plan_create(fx_comm* c, int world, const int64_t* numels, int 
     const int shards = (algo == FX_ALGO_ONE_SHOT) ? 1 : world;
     const long long slice_align = FX_SLICE_ALIGN / (long long)wsize;
     const size_t slice_target = (size_t)env_ll("FLASHY_B200_SLICE_BYTES", 8 << 10);
-    int max_blocks = c && !c->host_only ? c->max_blocks : 148;
+    int max_blocks = c && !c->host_only ? c->max_blocks : 132;     // dry plans: one CTA per SM of an H100 SXM
     if (c && c->plan_blocks > 0 && c->plan_blocks < max_blocks) max_blocks = c->plan_blocks;
     const long long per_shard = std::max<long long>((cur + shards - 1) / shards, 1);
     long long grid = (long long)(((size_t)per_shard * wsize + slice_target - 1) / slice_target);
@@ -908,16 +909,15 @@ extern "C" int fx_plan_create(fx_comm* c, int world, const int64_t* numels, int 
     p->shard = p->slice * grid;
     p->padded = p->shard * shards;
     p->wire_bytes = (size_t)p->padded * wsize;
-    // Pipelined kernel (pack / reduce / gather as concurrent warp roles).  Measured at 8 GPUs: it
-    // wins on many-tensor buckets (the per-tensor latency chains of pack and unpack hide behind
-    // the NVLink phase: ResNet-18 bf16 123 -> 110 us with NVLS) and on flat buffers from ~48 MiB,
-    // loses a few us below that, and loses when all ranks share one GPU (HBM-bound, roles compete).
+    // Pipelined kernel (pack / reduce / gather as concurrent warp roles).  The per-tensor latency chains
+    // of pack and unpack can hide behind the NVLink phase; when all ranks share one GPU the roles compete
+    // for HBM instead.  The auto rule below (NVLS buckets of >= 8 tensors or >= 48 MiB, never with
+    // virtual ranks) was tuned on an earlier target (B200) and is not yet re-measured on H100.
     // FLASHY_B200_PIPE: 0 never, 1 auto (default), 2 always.
     const long long pipe_mode = env_ll("FLASHY_B200_PIPE", 1);
     const bool pipe_able = algo != FX_ALGO_ONE_SHOT && dtype != FX_U8 &&
                            (wire_dtype == FX_F32 || wire_dtype == FX_BF16 || wire_dtype == FX_F16);
-    // (on the peer-to-peer path the roles starve each other: ResNet-18 bf16 137 -> 156 us at W = 8,
-    //  so auto mode pipelines NVLS buckets only)
+    // (on that target the roles starved each other on the peer-to-peer path, so auto mode pipelines NVLS buckets only)
     const bool pipe_auto = algo == FX_ALGO_NVLS && (n >= 8 || p->wire_bytes >= ((size_t)48 << 20)) && !(c && c->n_local > 1);
     if (pipe_able && (pipe_mode == 2 || (pipe_mode == 1 && pipe_auto))) {
         const long long chunk_target = env_ll("FLASHY_B200_CHUNK_BYTES", 4096) / (long long)wsize;
@@ -939,9 +939,8 @@ extern "C" int fx_plan_create(fx_comm* c, int world, const int64_t* numels, int 
         if (fx_fuse_smem_bytes(world, cbytes) <= (size_t)(192 << 10)) {
             p->fuse_chunk = cbytes / (long long)wsize;
             // Multimem vectors in flight per lane.  A rank reduces N / W bytes, so the depth the links need shrinks
-            // with the world: 1 (2 KiB per SM) is best at 8 GPUs (ResNet-50 fp32 bucket 279 us against 296 / 294 / 296
-            // for 2 / 4 / 8, profiles/r02_sync_n8_variants.jsonl), at 2 GPUs 1 loses a third against 8
-            // (546 vs 365 us, profiles/r02_raw/).
+            // with the world.  The 1 / 2 / 4 defaults per world size were tuned on an earlier target (B200) and are
+            // not yet re-measured on H100 (benchmarks/allreduce_sweep.py --variants compares them).
             const long long auto_depth = world >= 8 ? 1 : (world >= 4 ? 2 : 4);
             const long long depth = env_ll("FLASHY_B200_FUSE_DEPTH", auto_depth);
             p->fuse_unroll = (depth == 1 || depth == 2 || depth == 4 || depth == 8) ? (int)depth : (int)auto_depth;

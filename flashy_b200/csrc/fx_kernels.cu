@@ -1,10 +1,10 @@
-// Collective kernels for sm_100a: bucketed all-reduce (one-shot / two-shot over peer-mapped
+// Collective kernels for sm_90a (H100): bucketed all-reduce (one-shot / two-shot over peer-mapped
 // arenas), bucketed broadcast, local unpack and a device barrier.
 //
 // Replaces the per-tensor NCCL all-reduce + per-tensor divide loop of the reference
 // (flashy/distrib.py:105-111, :122-127, :174-190).  The path is an elementwise reduction: it
 // is bound by NVLink (W > 1 GPUs) or HBM (virtual ranks on one GPU), never by the tensor
-// cores, so there is no tcgen05 here -- only 128-bit coalesced global/peer accesses, release /
+// cores, so there is no wgmma here -- only 128-bit coalesced global/peer accesses, release /
 // acquire flags at system scope, and fp32 accumulation in registers.
 //
 // Data flow of the two-shot kernel, for hosted rank r and CTA b (every CTA owns slice b of

@@ -1,4 +1,4 @@
-"""Blackwell-native drop-in for ``flashy.distrib`` (reference: ``flashy/distrib.py``).
+"""Hopper-native (H100) drop-in for ``flashy.distrib`` (reference: ``flashy/distrib.py``).
 
 Same names, signatures, in-place semantics and error behaviour as the reference module; the
 body is new.  Where the reference issues one ``torch.distributed`` collective and one divide
@@ -424,9 +424,9 @@ def _average(ctx, todo: tp.List[torch.Tensor]) -> None:
     else:
         key = _list_key(todo)
         known = ("ar", key, engine.wire_bf16) in engine.layouts
-        if engine.host_only:
-            _check_number_of_params(todo, key)
-            _flat(todo[0], -1)                     # raises: no CPU fallback
+        if engine.host_only or not all(t.is_cuda for t in todo):
+            _check_number_of_params(todo, key)     # as in the reference, the count check comes first
+            _dense_or_raise(todo)                  # raises: no CPU fallback
         layout = _layout_for(ctx, engine, "ar", todo, N.FX_AVG, key, lossy=True)
         engine.fast_lists[slot] = _ListEntry(numels, [t.dtype for t in todo], key, layout)
         if len(engine.fast_lists) > 64:
@@ -532,7 +532,7 @@ torch.nn.modules.module.register_module_buffer_registration_hook(_bump_struct_ep
 
 def _model_entry(model: torch.nn.Module) -> _ModelLists:
     """``list(model.parameters())`` / ``list(model.buffers())`` walk the whole module tree on
-    every call (~100 us for ResNet-18 -- more than the all-reduce itself takes on NVLink), so
+    every call (for ResNet-18 a cost of the order of the all-reduce itself), so
     the lists are cached per model.  The cache is dropped whenever any module's structure was
     edited since it was taken (``_struct_epoch``), and re-derived every 256 uses as a backstop for
     edits that bypass the registration API (``del model.fc``, writes to ``_parameters``)."""
@@ -573,9 +573,9 @@ def _average_cached(ctx, entry: _ModelLists, tag: str, todo: tp.List[torch.Tenso
         fresh = False
     else:
         key = _list_key(todo)
-        if engine.host_only:
+        if engine.host_only or not all(t.is_cuda for t in todo):
             _check_number_of_params(todo, key)
-            _flat(todo[0], -1)
+            _dense_or_raise(todo)
         layout = _layout_for(ctx, engine, "ar", todo, N.FX_AVG, key, lossy=True)
         entry.fast[slot] = (key, layout)
         fresh = True
@@ -732,7 +732,7 @@ class _Overlap:
                 or any(b.plan.handle is None for b in cached[1].buckets):
             key = _list_key(tensors)
             # buckets launched DURING backward run on a small grid (FLASHY_B200_OVERLAP_BLOCKS, 32): every CTA of
-            # the fused kernel takes a whole SM's shared memory, and 148 of them would lock backward out.  What
+            # the fused kernel takes a whole SM's shared memory, and one per SM would lock backward out.  What
             # sync_model itself sends (tail, held-back buckets) is exposed anyway and uses the full grid.
             engine.plan_blocks = self.blocks if tag[0] == "hook" else 0
             try:

@@ -14,7 +14,7 @@ Two restatements of the reference path live here:
   CPU baseline.
 
 Pinning: both are checked by ``tests/test_oracle.py`` against ``tests/golden/*.npz``,
-which were produced by importing the *unmodified* ``/root/reference/flashy/distrib.py``
+which were produced by importing the *unmodified* reference ``flashy/distrib.py``
 in the build container and running it over gloo with 2, 4 and 8 processes
 (``tests/golden/make_golden.py``), and against the known answers of the reference's own
 ``tests/test_distrib.py`` (mean of 1..8 == 4.5 exactly, broadcast == 1.0 exactly,

@@ -1,18 +1,17 @@
 """CPU baseline of the benchmark workload (TEST / BENCH INFRASTRUCTURE, never shipped).
 
-Runs the reference's training step of ``examples/cifar`` (``/root/reference/examples/cifar/
-solver.py:46-53``: forward, cross-entropy, backward, ``distrib.sync_model``, ``optim.step``,
+Runs the reference's training step of ``examples/cifar`` (``examples/cifar/solver.py:46-53``
+of the reference: forward, cross-entropy, backward, ``distrib.sync_model``, ``optim.step``,
 ``optim.zero_grad``) on the host cores: W processes over gloo, the gradient sync being the
 reference's own call sequence as restated in ``oracle/refdistrib.py`` (one all-reduce and one
 divide per tensor, two host-synchronising count checks).  Used by ``bench.py`` for the
 ``cpu_baseline`` object and for ``--impl reference``.
 
-Placement (measured on the GPU box's 128-core host, ``benchmarks/cpu_baseline_variants.py`` ->
-``profiles/r02_cpu_baseline_variants.jsonl``): with OpenMP's default ACTIVE wait policy the idle
-workers of 8 x 16 threads spin on the very cores gloo's transport threads need -- 160 samples/s
-pinned, 387 unpinned, and a 4.6x spread between two boxes in round 1.  With a PASSIVE wait policy
-(``OMP_WAIT_POLICY=passive``, ``GOMP_SPINCOUNT=0``) the same job runs at 1 430 - 1 450 samples/s.
-The default is therefore the fastest stable configuration found: every rank pinned to its own
+Placement (``benchmarks/cpu_baseline_variants.py`` compares the options on a given host): with
+OpenMP's default ACTIVE wait policy the idle workers of W x (cores / W) threads spin on the very
+cores gloo's transport threads need, which makes the baseline several times slower and unstable
+from host to host.  A PASSIVE wait policy (``OMP_WAIT_POLICY=passive``, ``GOMP_SPINCOUNT=0``)
+avoids that.  The default is therefore the fastest stable configuration found: every rank pinned to its own
 disjoint core set (``os.sched_setaffinity``), one core of the set left to the transport, passive
 waiting; the reported step time is the MEDIAN over the timed steps of the per-step max over ranks,
 and the rendezvous is an explicit ``tcp://`` store so that a surrounding ``torch.distributed.run``

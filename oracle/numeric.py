@@ -1,7 +1,7 @@
 """Single-process arithmetic model of the reference's collectives (TEST INFRASTRUCTURE).
 
 Every function takes the inputs of *all* W ranks (index 0 = rank 0) and returns what the
-reference leaves in each rank's tensors.  Citations are into /root/reference/.
+reference leaves in each rank's tensors.  Citations are into the reference checkout (facebookresearch/flashy).
 
 Arithmetic contract restated from ``flashy/distrib.py``:
 

@@ -1,6 +1,6 @@
 """The reference's collective call sequence over ``torch.distributed`` (TEST INFRASTRUCTURE).
 
-A behavioural restatement -- not a copy -- of ``/root/reference/flashy/distrib.py``: for each
+A behavioural restatement -- not a copy -- of the reference's ``flashy/distrib.py``: for each
 public function of the hot path, the same collectives in the same order with the same
 host synchronisation points, issued through whatever process group ``torch.distributed``
 was initialised with (gloo on CPU here; NCCL on a GPU box).  It serves as

@@ -11,7 +11,7 @@ os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # The product has no fallback when libflashy_b200.so is missing; build it (nvcc cross-compiles
     # without a GPU) so that a fresh checkout can run the suite directly.
     if not (ROOT / "flashy_b200" / "libflashy_b200.so").exists():

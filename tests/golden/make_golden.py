@@ -1,11 +1,12 @@
 """Generate tests/golden/ref_w{2,4,8}.npz by running the UNMODIFIED reference.
 
-Run in the build container only (``/root/reference`` does not exist on the GPU box):
+Needs a checkout of the reference (``$FLASHY_REFERENCE``, else ``/root/reference``, as for
+``oracle/install_ref.py``); the tests only read the stored .npz files:
 
-    python tests/golden/make_golden.py
+    FLASHY_REFERENCE=<checkout> python tests/golden/make_golden.py
 
-``/root/reference/flashy/distrib.py`` is loaded as-is with ``importlib`` (the package's
-``__init__`` cannot be imported: ``dora``/``colorlog`` are absent and uninstallable here);
+The checkout's ``flashy/distrib.py`` is loaded as-is with ``importlib`` (the package's
+``__init__`` cannot be imported: ``dora``/``colorlog`` are not installed);
 the only stand-in is a three-function ``dora.distrib`` module (``rank``, ``world_size``,
 ``init``) placed in ``sys.modules`` before the import, exactly as SURVEY.md appendix A.1
 describes.  Every value in the .npz files is therefore an output of the reference's own
@@ -30,7 +31,7 @@ HERE = Path(__file__).resolve().parent
 sys.path.insert(0, str(HERE))
 import cases  # noqa: E402
 
-REFERENCE = Path("/root/reference/flashy/distrib.py")
+REFERENCE = Path(os.environ.get("FLASHY_REFERENCE") or "/root/reference") / "flashy" / "distrib.py"
 
 
 def load_reference():
@@ -169,7 +170,7 @@ def run_rank(rank: int, world: int, port: int, out_path: str):
 
 
 def main():
-    assert REFERENCE.exists(), "run this in the build container (needs /root/reference)"
+    assert REFERENCE.exists(), f"{REFERENCE} not found: set FLASHY_REFERENCE to a checkout of the reference"
     ctx = mp.get_context("spawn")
     for world in cases.WORLDS:
         port = random.randrange(30000, 40000)

@@ -3,7 +3,7 @@
 Same golden vectors / oracle as tests/test_gpu_parity.py, but the ranks are real processes
 whose arenas are exchanged through the C ABI bootstrap (VMM fd passing or cudaIpc); also the
 hybrid layout (2 processes x 2 virtual ranks).  Skipped on a one-GPU box; run with
-``gpurun --gpus 2|4|8 -- python -m pytest tests/test_gpu_multiproc.py -m gpu``.
+``python -m pytest tests/test_gpu_multiproc.py -m gpu`` on a machine with 2, 4 or 8 GPUs.
 """
 import numpy as np
 import pytest

@@ -1,7 +1,7 @@
 """More of the one-process-per-GPU layout (needs >= 2 GPUs): the cudaIpc memory path
 (``FLASHY_B200_MEM=ipc``), ``FLASHY_B200_CHECK=plan``, ``distrib.wrap`` (the DDP comparator the reference
 keeps, ``flashy/distrib.py:65-75``) and plan-cache eviction with real processes.
-``gpurun --gpus 2 -- python -m pytest tests/test_gpu_multiproc_extra.py -m gpu``."""
+``python -m pytest tests/test_gpu_multiproc_extra.py -m gpu`` on a machine with 2 GPUs."""
 import pytest
 import torch
 from torch import nn

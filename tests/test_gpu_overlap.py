@@ -1,6 +1,6 @@
 """Backward overlap for plain ``sync_model`` users (SURVEY.md 8(f) rank 1, second half; reference anchor
 ``flashy/distrib.py:193-224``), one process per GPU (needs >= 2 GPUs):
-``gpurun --gpus 2 -- python -m pytest tests/test_gpu_overlap.py -m gpu``.
+``python -m pytest tests/test_gpu_overlap.py -m gpu`` on a machine with 2 or more GPUs.
 
 Every rank can rebuild every rank's seeded batch, so each process computes all per-rank gradients
 locally and averages them with the oracle (``oracle/numeric.py``); the overlapped ``sync_model`` must

@@ -48,7 +48,7 @@ def run(world, fn, *args):
 
 # --------------------------------------------------------------------------- reference's own test
 def test_reference_test_distrib_on_cuda():
-    """/root/reference/tests/test_distrib.py:26-79, same assertions, CUDA tensors, WS = 8."""
+    """The reference's tests/test_distrib.py:26-79, same assertions, CUDA tensors, WS = 8."""
     from collections import defaultdict
     from torch import nn
     from flashy_b200 import distrib

@@ -1,7 +1,7 @@
 """Pin the oracle (oracle/numeric.py, oracle/refdistrib.py) to the unmodified reference.
 
 Golden vectors: tests/golden/ref_w{2,4,8}.npz, produced by tests/golden/make_golden.py from
-/root/reference/flashy/distrib.py over gloo.  Known answers: reference tests/test_distrib.py:29-46.
+the reference's flashy/distrib.py over gloo.  Known answers: reference tests/test_distrib.py:29-46.
 """
 import numpy as np
 import pytest
