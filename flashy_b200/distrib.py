@@ -357,6 +357,8 @@ _OPS = {
     distributed.ReduceOp.MAX: N.FX_MAX, distributed.ReduceOp.MIN: N.FX_MIN,
     distributed.ReduceOp.PRODUCT: N.FX_PROD,
 }
+_NO_COMPLEX_OPS = (distributed.ReduceOp.MAX, distributed.ReduceOp.MIN, distributed.ReduceOp.PRODUCT,
+                   distributed.ReduceOp.BAND, distributed.ReduceOp.BOR, distributed.ReduceOp.BXOR)
 
 
 def all_reduce(tensor: torch.Tensor, op=distributed.ReduceOp.SUM):
@@ -364,6 +366,10 @@ def all_reduce(tensor: torch.Tensor, op=distributed.ReduceOp.SUM):
     ctx = _context.current()
     if ctx.world == 1:
         return None
+    # torch.distributed.all_reduce refuses these on complex tensors (distributed_c10d.supports_complex):
+    # reduced as independent (re, im) pairs they would be silently wrong (PRODUCT most of all).
+    if tensor.is_complex() and op in _NO_COMPLEX_OPS:
+        raise ValueError(f"all_reduce does not support {op} on complex tensors")
     fx_op = _OPS.get(op)
     if fx_op is None:
         raise RuntimeError(f"reduce op {op} is not supported by flashy_b200")

@@ -131,6 +131,36 @@ def test_virtual_ranks_host_logic():
     assert distrib.world_size() == 1      # outside the virtual world again
 
 
+def test_all_reduce_refuses_order_ops_on_complex():
+    """MAX / MIN / PRODUCT of complex tensors raise ValueError on every rank, as torch.distributed
+    does, before any rendezvous and before the data path refuses CPU tensors; SUM / AVG do not."""
+    from flashy_b200 import VirtualWorld, distrib
+    from torch.distributed import ReduceOp
+    vw = VirtualWorld(2)
+
+    def body(rank, w):
+        seen = []
+        for dtype in (torch.complex64, torch.complex128):
+            x = torch.full((3,), 1 + 2j, dtype=dtype)
+            for op in (ReduceOp.MAX, ReduceOp.MIN, ReduceOp.PRODUCT):
+                with pytest.raises(ValueError) as err:
+                    distrib.all_reduce(x, op)
+                seen.append(str(err.value))
+            assert torch.equal(x, torch.full((3,), 1 + 2j, dtype=dtype))
+        if vw.engine.host_only:               # SUM still reaches the data path, which has no CPU fallback
+            with pytest.raises(RuntimeError, match="CPU fallback"):
+                distrib.all_reduce(torch.ones(3, dtype=torch.complex64), ReduceOp.SUM)
+        return seen
+
+    try:
+        got = vw.run(body)
+    finally:
+        vw.close()
+    want = [f"all_reduce does not support {op} on complex tensors"
+            for _ in range(2) for op in (ReduceOp.MAX, ReduceOp.MIN, ReduceOp.PRODUCT)]
+    assert got == [want, want]
+
+
 def _abort_worker(rank, world):
     """A rank that fails poisons the communicator: the others error out promptly, nobody hangs."""
     import time

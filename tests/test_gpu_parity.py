@@ -259,7 +259,7 @@ def test_resnet18_bucket_vs_oracle(dtype):
         for g, w_ in zip(got[r], want):
             assert torch.equal(g, w_)
     big = [p.info for p in vworld(world).engine.plans.values() if p.info.wire_bytes > (4 << 20)]
-    assert big and all(p.algo == 2 for p in big)                # two-shot path was the one exercised
+    assert big and all(p.algo == 2 and p.kernel == 6 for p in big)   # sharded: k_fuse<NVLS=false> ran
 
 
 def test_size_independent_properties_at_full_size():
@@ -483,10 +483,12 @@ def test_count_mismatch_raises_on_every_rank_cuda():
 
 @pytest.mark.parametrize("dtype", (torch.bfloat16, torch.float32))
 def test_pipelined_kernel_forced_in_loopback(monkeypatch, dtype):
-    """The warp-role pipelined kernel (default on real multi-GPU buckets) forced on for virtual
-    ranks, with small chunks so that every CTA runs several pipeline stages."""
+    """The warp-role pipelined kernel (k_pipe<NVLS=false>) forced on for virtual ranks, with small
+    chunks so that every CTA runs several pipeline stages.  The fused kernel, which the planner
+    prefers whenever it is enabled, is switched off."""
     from flashy_b200 import VirtualWorld, distrib
     import torchvision
+    monkeypatch.setenv("FLASHY_B200_FUSE", "0")
     monkeypatch.setenv("FLASHY_B200_PIPE", "2")
     monkeypatch.setenv("FLASHY_B200_CHUNK_BYTES", "2048")
     world = 8
@@ -510,6 +512,8 @@ def test_pipelined_kernel_forced_in_loopback(monkeypatch, dtype):
         for r in range(world):
             for g, w_ in zip(got[r], want):
                 assert torch.equal(g, w_)
+        kernels = [int(p.info.kernel) for p in vw.engine.plans.values()]
+        assert kernels and all(k == 4 for k in kernels), kernels      # k_pipe<NVLS=false>
     finally:
         vw.close()
 
