@@ -33,7 +33,7 @@ EXPORTS = (
     "fx_comm_get_info", "fx_comm_set_plan_blocks", "fx_comm_get_pointers", "fx_comm_trace_read", "fx_comm_poll", "fx_comm_abort", "fx_comm_destroy",
     "fx_host_exchange", "fx_host_barrier", "fx_host_broadcast",
     "fx_plan_create", "fx_plan_get_info", "fx_plan_offsets", "fx_plan_destroy",
-    "fx_allreduce", "fx_broadcast", "fx_allreduce_begin", "fx_allreduce_finish", "fx_barrier",
+    "fx_allreduce", "fx_allreduce_hosted", "fx_broadcast", "fx_allreduce_begin", "fx_allreduce_finish", "fx_barrier",
 )
 
 
@@ -93,6 +93,7 @@ def _load() -> C.CDLL:
         "fx_plan_offsets": (i, [vp, P(C.c_int64)]),
         "fx_plan_destroy": (None, [vp]),
         "fx_allreduce": (i, [vp, i, P(vp), P(vp), vp]),
+        "fx_allreduce_hosted": (i, [vp, i, i, i, C.c_int64, u64, P(vp), P(vp), vp, vp, P(C.c_int64), P(i)]),
         "fx_broadcast": (i, [vp, i, P(vp), vp]),
         "fx_allreduce_begin": (i, [vp, i, P(vp), vp]),
         "fx_allreduce_finish": (i, [vp, P(vp), vp]),

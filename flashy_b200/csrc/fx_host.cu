@@ -725,6 +725,9 @@ extern "C" void fx_comm_destroy(fx_comm* c) {
         for (int r = 0; r < c->world; ++r) arena_release(c, c->arena[r]);
         if (c->status_host) cudaFreeHost(c->status_host);
         if (c->order_event) cudaEventDestroy(c->order_event);
+        for (int l = 0; l < c->n_local; ++l)
+            if (c->rank_event[l]) cudaEventDestroy(c->rank_event[l]);
+        if (c->hosted_done) cudaEventDestroy(c->hosted_done);
         if (c->trace_dev) cudaFree(c->trace_dev);
         cudaGetLastError();
     }
@@ -996,6 +999,8 @@ extern "C" int fx_plan_create(fx_comm* c, int world, const int64_t* numels, int 
         }
         p->h_in.assign(nptr, nullptr);
         p->h_out.assign(nptr, nullptr);
+        p->row_in.assign(nptr, nullptr);
+        p->row_out.assign(nptr, nullptr);
     }
     *out = p;
     return FX_OK;
@@ -1164,13 +1169,9 @@ static int pre_launch(fx_comm* c, fx_plan* p, cudaStream_t stream) {
     return FX_OK;
 }
 
-extern "C" int fx_allreduce(fx_plan* p, int op, const void* const* in_ptrs, void* const* out_ptrs, void* stream) {
-    if (!p || !in_ptrs || !out_ptrs) return fx_fail(FX_ERR_INVALID, "NULL argument");
-    fx_comm* c = p->comm;
-    if (!c) return fx_fail(FX_ERR_STATE, "dry plan cannot be launched");
-    if (!fx_kernel_supported(p->dtype, p->wire, op, false)) return fx_fail(FX_ERR_UNSUPPORTED, "all-reduce op %d on dtype %d is not supported", op, p->dtype);
-    std::lock_guard<std::mutex> lock(c->mu);
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
+// The launch of fx_allreduce; the caller holds c->mu.
+static int allreduce_locked(fx_comm* c, fx_plan* p, int op, const void* const* in_ptrs, void* const* out_ptrs,
+                            cudaStream_t s) {
     int rc = pre_launch(c, p, s);
     if (rc != FX_OK) return rc;
     const size_t nptr = (size_t)c->n_local * p->n;
@@ -1188,6 +1189,125 @@ extern "C" int fx_allreduce(fx_plan* p, int op, const void* const* in_ptrs, void
     }
     if (rc == FX_OK) c->launches++;
     return rc;
+}
+
+extern "C" int fx_allreduce(fx_plan* p, int op, const void* const* in_ptrs, void* const* out_ptrs, void* stream) {
+    if (!p || !in_ptrs || !out_ptrs) return fx_fail(FX_ERR_INVALID, "NULL argument");
+    fx_comm* c = p->comm;
+    if (!c) return fx_fail(FX_ERR_STATE, "dry plan cannot be launched");
+    if (!fx_kernel_supported(p->dtype, p->wire, op, false)) return fx_fail(FX_ERR_UNSUPPORTED, "all-reduce op %d on dtype %d is not supported", op, p->dtype);
+    std::lock_guard<std::mutex> lock(c->mu);
+    return allreduce_locked(c, p, op, in_ptrs, out_ptrs, static_cast<cudaStream_t>(stream));
+}
+
+// Wait until the launcher of collective `epoch` has published it; same spin / yield / sleep policy as
+// host_wait_all, and the same abort and timeout rules.
+static int hosted_wait(fx_comm* c, long long epoch, double timeout_s) {
+    const double t0 = now_s();
+    unsigned spins = 0;
+    while (c->hosted_epoch.load(std::memory_order_acquire) < epoch) {
+        if (++spins < 2000) continue;
+        sched_yield();
+        if ((spins & 0xff) == 0) {
+            if (c->shm->aborted.load(std::memory_order_acquire))
+                return fx_fail(FX_ERR_STATE, "hosted all-reduce: the communicator was aborted by a rank that failed");
+            if (now_s() - t0 > timeout_s)
+                return fx_fail(FX_ERR_TIMEOUT, "hosted all-reduce: a hosted rank did not arrive within %.0f s (collective #%lld)",
+                               timeout_s, epoch);
+            if (spins > 200000) usleep(50);
+        }
+    }
+    return FX_OK;
+}
+
+extern "C" int fx_allreduce_hosted(fx_plan* p, int local, int op, int check, int64_t count, uint64_t signature,
+                                   const void* const* in_row, void* const* out_row, void* rank_stream,
+                                   void* launch_stream, int64_t* sum_out, int* sig_equal) {
+    if (!p || !in_row || !out_row) return fx_fail(FX_ERR_INVALID, "NULL argument");
+    fx_comm* c = p->comm;
+    if (!c) return fx_fail(FX_ERR_STATE, "dry plan cannot be launched");
+    if (c->host_only || !c->connected || !c->shm) return fx_fail(FX_ERR_STATE, "this communicator has no connected device side");
+    if (local < 0 || local >= c->n_local) return fx_fail(FX_ERR_INVALID, "bad local index %d", local);
+    if (!fx_kernel_supported(p->dtype, p->wire, op, false)) return fx_fail(FX_ERR_UNSUPPORTED, "all-reduce op %d on dtype %d is not supported", op, p->dtype);
+    if (c->shm->aborted.load(std::memory_order_acquire)) return fx_fail(FX_ERR_STATE, "the communicator was aborted by a rank that failed");
+    cudaStream_t rs = static_cast<cudaStream_t>(rank_stream);
+    FX_CUDA(cudaSetDevice(c->device));
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    FX_CUDA(cudaStreamIsCapturing(rs, &cap));
+    if (cap != cudaStreamCaptureStatusNone)
+        return fx_fail(FX_ERR_STATE, "fx_allreduce_hosted cannot be stream-captured: use fx_allreduce");
+
+    // ---- before arriving: this rank's pointer row, its stream, and the stream's state
+    const size_t n = (size_t)p->n;
+    memcpy(&p->row_in[(size_t)local * n], in_row, n * sizeof(void*));
+    memcpy(&p->row_out[(size_t)local * n], out_row, n * sizeof(void*));
+    c->hosted_stream[local] = rank_stream;
+    if (!c->rank_event[local]) FX_CUDA(cudaEventCreateWithFlags(&c->rank_event[local], cudaEventDisableTiming));
+    FX_CUDA(cudaEventRecord(c->rank_event[local], rs));
+
+    // ---- count check over every rank of the world (all processes), before anything is launched
+    if (check) {
+        int64_t sum = 0;
+        int equal = 0;
+        int rc = fx_host_exchange(c, local, count, signature, &sum, &equal, 0.0);
+        if (rc != FX_OK) return rc;
+        if (sum_out) *sum_out = sum;
+        if (sig_equal) *sig_equal = equal;
+        if (sum != count * c->world || !equal)
+            return fx_fail(FX_ERR_MISMATCH, "count check failed: %lld tensors over the world, %lld expected; signatures %s",
+                           (long long)sum, (long long)(count * c->world), equal ? "agree" : "differ");
+    }
+
+    // ---- arrive; the last hosted rank to arrive launches.  The epoch cannot move before this rank arrives,
+    // so the value read here is the one the launcher of this collective will advance.
+    const long long epoch = c->hosted_epoch.load(std::memory_order_acquire) + 1;
+    const bool launcher = c->hosted_arrived.fetch_add(1, std::memory_order_acq_rel) + 1 == c->n_local;
+    if (launcher) {
+        int rc = FX_OK;
+        {
+            std::lock_guard<std::mutex> lock(c->mu);
+            bool shared = true;
+            for (int l = 1; l < c->n_local; ++l) shared = shared && c->hosted_stream[l] == c->hosted_stream[0];
+            // All ranks on one stream: launch on it, it already orders everything.  Otherwise the launch stream
+            // waits for every rank's stream and the ranks wait for `hosted_done`.  Reusing one `hosted_done`
+            // event is safe: every rank enqueues its wait on it before it returns from this call, hence before it
+            // can arrive at the next collective, and the next launcher records it only after all have arrived.
+            // The same argument covers the rank events, which a rank records again only after this launch.
+            cudaStream_t ls = shared ? static_cast<cudaStream_t>(c->hosted_stream[0]) : static_cast<cudaStream_t>(launch_stream);
+            if (!shared) {
+                for (int l = 0; l < c->n_local && rc == FX_OK; ++l) {
+                    bool seen = false;
+                    for (int q = 0; q < l; ++q) seen = seen || c->hosted_stream[q] == c->hosted_stream[l];
+                    if (!seen && cudaStreamWaitEvent(ls, c->rank_event[l], 0) != cudaSuccess)
+                        rc = fx_fail(FX_ERR_CUDA, "cudaStreamWaitEvent(rank %d): %s", l, cudaGetErrorString(cudaGetLastError()));
+                }
+            }
+            if (rc == FX_OK) rc = allreduce_locked(c, p, op, p->row_in.data(), p->row_out.data(), ls);
+            if (rc == FX_OK && !shared && !c->hosted_done) {
+                if (cudaEventCreateWithFlags(&c->hosted_done, cudaEventDisableTiming) != cudaSuccess)
+                    rc = fx_fail(FX_ERR_CUDA, "cudaEventCreate: %s", cudaGetErrorString(cudaGetLastError()));
+            }
+            if (rc == FX_OK && !shared && cudaEventRecord(c->hosted_done, ls) != cudaSuccess)
+                rc = fx_fail(FX_ERR_CUDA, "cudaEventRecord(done): %s", cudaGetErrorString(cudaGetLastError()));
+            c->hosted_join = !shared;
+        }
+        c->hosted_rc = rc;
+        if (rc != FX_OK) {
+            memcpy(c->hosted_err, g_err, sizeof(c->hosted_err) - 1);     // g_err is longer and NUL-terminated
+            c->hosted_err[sizeof(c->hosted_err) - 1] = 0;
+        }
+        c->hosted_arrived.store(0, std::memory_order_relaxed);
+        c->hosted_epoch.store(epoch, std::memory_order_release);
+    } else {
+        int rc = hosted_wait(c, epoch, env_double("FLASHY_B200_HOST_TIMEOUT", 600.0));
+        if (rc != FX_OK) return rc;
+    }
+    if (c->hosted_rc != FX_OK) {
+        if (!launcher) fx_fail(c->hosted_rc, "%s", c->hosted_err);
+        return c->hosted_rc;
+    }
+    if (c->hosted_join) FX_CUDA(cudaStreamWaitEvent(rs, c->hosted_done, 0));
+    return FX_OK;
 }
 
 int fx_plan_kernel_id(const fx_plan* p, int op) {

@@ -129,6 +129,15 @@ struct fx_comm {
     bool have_last = false;
     cudaEvent_t order_event = nullptr;
     unsigned long long* trace_dev = nullptr;    // FLASHY_B200_TRACE=1: per-role time stamps of the fused kernel
+    // fx_allreduce_hosted: the hosted ranks of this process meet here, and the last to arrive launches
+    cudaEvent_t rank_event[FX_MAX_WORLD] = {nullptr};   // per hosted rank: its stream's state at arrival
+    cudaEvent_t hosted_done = nullptr;                  // the launch stream after the launch
+    void* hosted_stream[FX_MAX_WORLD] = {nullptr};      // per hosted rank: its stream of the current collective
+    std::atomic<int> hosted_arrived{0};                 // hosted ranks arrived at the current collective
+    std::atomic<long long> hosted_epoch{0};             // collectives launched (published by the launcher)
+    int hosted_rc = FX_OK;                              // the launcher's return code, valid once the epoch moved
+    bool hosted_join = false;                           // the ranks must wait on hosted_done
+    char hosted_err[512] = {0};                         // the launcher's error message when hosted_rc != FX_OK
 };
 
 struct fx_plan {
@@ -153,6 +162,8 @@ struct fx_plan {
     FxPlanState* d_state = nullptr;
     std::vector<const void*> h_in;
     std::vector<void*> h_out;
+    std::vector<const void*> row_in;            // fx_allreduce_hosted: each hosted rank writes its row here
+    std::vector<void*> row_out;
     bool in_valid = false, out_valid = false;
     bool begun = false;
     bool captured = false;                      // a launch of this plan was stream-captured (see upload_ptrs)

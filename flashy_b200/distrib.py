@@ -16,6 +16,7 @@ Environment knobs (none of them changes a public signature):
 ``FLASHY_B200_ONE_SHOT_MAX`` (bytes, 262144), ``FLASHY_B200_SLICE_BYTES`` (8192),
 ``FLASHY_B200_WIRE=bf16`` (send fp32 gradients as bf16: opt-in, lossy, averaged gradients only),
 ``FLASHY_B200_CHECK=always|plan`` (count check every call, or only when a bucket plan is new),
+``FLASHY_B200_HOSTED_LAUNCH=0`` (virtual ranks meet in a Python rendezvous instead of ``fx_allreduce_hosted``; for A/B runs),
 ``FLASHY_B200_OVERLAP=1`` / ``FLASHY_B200_OVERLAP_BUCKET_MB`` (8) / ``FLASHY_B200_OVERLAP_TAIL_KB`` (512) /
 ``FLASHY_B200_OVERLAP_BLOCKS`` (32): backward overlap for ``sync_model`` (see ``overlap``; an addition, off by default).
 """
@@ -143,6 +144,15 @@ def _key_signature(key) -> int:
     return hash(key) & (2 ** 64 - 1)          # tuples of ints: independent of PYTHONHASHSEED
 
 
+def _raise_on_mismatch(count: int, total: int, same: bool, world: int) -> None:
+    if total != count * world:
+        raise RuntimeError(f"Mismatch in number of params: ours is {count}, "
+                           "at least one worker has a different one.")
+    if not same:
+        raise RuntimeError("Mismatch in the shapes/dtypes of the tensors to synchronise: "
+                           "at least one worker passed a different list.")
+
+
 def _check_number_of_params(params: tp.Sequence[torch.Tensor], key=None) -> None:
     """Reference flashy/distrib.py:78-89, without its device all-reduce and ``.item()`` sync:
     the counts meet in host shared memory.  Raises on EVERY rank if any rank differs."""
@@ -152,12 +162,15 @@ def _check_number_of_params(params: tp.Sequence[torch.Tensor], key=None) -> None
     engine = _engine(ctx, params)
     sig = _key_signature(key if key is not None else _list_key(params))
     total, same = engine.host_exchange(ctx.local, len(params), sig)
-    if total != len(params) * ctx.world:
-        raise RuntimeError(f"Mismatch in number of params: ours is {len(params)}, "
-                           "at least one worker has a different one.")
-    if not same:
-        raise RuntimeError("Mismatch in the shapes/dtypes of the tensors to synchronise: "
-                           "at least one worker passed a different list.")
+    _raise_on_mismatch(len(params), total, same, ctx.world)
+
+
+def _hosted(ctx, engine: Engine) -> bool:
+    """Whether this call's all-reduces go through ``fx_allreduce_hosted``: hosted ranks meet and launch
+    inside the library, without the GIL.  Stream capture (refused there) and ``engine.profile`` (whose
+    events must bracket the one launch) keep the Python rendezvous."""
+    return (ctx.n_local > 1 and engine.hosted_launch and not engine.host_only and not engine.profile
+            and not torch.cuda.is_current_stream_capturing())
 
 
 def _launch_streams(engine: Engine, payloads: tp.Sequence[tp.Any], launch: tp.Callable[[tp.Any], None]):
@@ -197,12 +210,32 @@ class _Bucket:
 
 class _Layout:
     """Bucket plan of one ordered tensor list (cached by dtype/numel signature)."""
-    __slots__ = ("kind", "buckets", "used", "last_in", "last_out", "fresh")
+    __slots__ = ("kind", "buckets", "used", "last_in", "last_out", "fresh", "rows")
 
     def __init__(self, kind, buckets, used):
         self.kind, self.buckets, self.used = kind, buckets, used
         self.last_in = self.last_out = None
         self.fresh = True
+        self.rows: tp.Dict[int, "_Rows"] = {}      # hosted rank -> its rows of the fx_allreduce_hosted launches
+
+
+class _Rows:
+    """One hosted rank's pointer rows of a layout: the address lists it launched last and, per bucket,
+    the ctypes arrays built from them (rebuilt only when an address moved)."""
+    __slots__ = ("last_in", "last_out", "in_arr", "out_arr")
+
+    def __init__(self, layout: _Layout):
+        self.last_in = self.last_out = None
+        self.in_arr = [(N.C.c_void_p * len(b.idx))() for b in layout.buckets]
+        self.out_arr = [(N.C.c_void_p * len(b.idx))() for b in layout.buckets]
+
+
+def _last_in(ctx, layout: _Layout) -> tp.Optional[tp.List[int]]:
+    """The input addresses this rank last launched ``layout`` with (None if unknown)."""
+    if ctx.n_local == 1:
+        return layout.last_in
+    rows = layout.rows.get(ctx.local)
+    return rows.last_in if rows is not None else None
 
 
 def split_buckets(items: tp.Sequence[tp.Tuple[int, int]], cap: int, esize: int
@@ -279,9 +312,40 @@ def _dense_or_raise(tensors: tp.Sequence[torch.Tensor], device: tp.Optional[int]
             raise ValueError("Tensors must be contiguous")
 
 
+def _run_hosted(ctx, engine: Engine, layout: _Layout, in_ptrs: tp.List[int], out_ptrs: tp.List[int], op: int,
+                check) -> None:
+    """Every bucket of an all-reduce layout through ``fx_allreduce_hosted``: one GIL-free native call per
+    bucket in which the hosted ranks meet and the last to arrive launches.  ``check`` = (count, key):
+    the count check, done by the first bucket's call before anything is launched."""
+    rows = layout.rows.get(ctx.local)
+    if rows is None:
+        rows = layout.rows[ctx.local] = _Rows(layout)
+    if in_ptrs != rows.last_in or out_ptrs != rows.last_out:
+        for b, ins, outs in zip(layout.buckets, rows.in_arr, rows.out_arr):
+            ins[:] = [in_ptrs[i] + o for i, o in zip(b.idx, b.off)]
+            outs[:] = [out_ptrs[i] + o for i, o in zip(b.idx, b.off)]
+        rows.last_in, rows.last_out = in_ptrs, out_ptrs
+    stream = torch.cuda.current_stream().cuda_stream
+    side = engine.side_stream.cuda_stream
+    total, same = N.C.c_int64(), N.C.c_int()
+    for k, b in enumerate(layout.buckets):
+        checked = check is not None and k == 0
+        count, sig = (check[0], _key_signature(check[1])) if checked else (0, 0)
+        rc = N.lib.fx_allreduce_hosted(b.plan.handle, ctx.local, op, int(checked), count, sig, rows.in_arr[k],
+                                       rows.out_arr[k], stream, side, N.C.byref(total), N.C.byref(same))
+        if rc == N.FX_ERR_MISMATCH and checked:
+            _raise_on_mismatch(count, total.value, bool(same.value), ctx.world)
+        if rc:
+            N.check(rc)
+
+
 def _run_layout(ctx, engine: Engine, layout: _Layout, in_ptrs: tp.List[int],
-                out_ptrs: tp.List[int], op: int, src: int = 0) -> None:
-    """Launch every bucket of ``layout`` on the tensors' current addresses."""
+                out_ptrs: tp.List[int], op: int, src: int = 0, hosted: bool = False, check=None) -> None:
+    """Launch every bucket of ``layout`` on the tensors' current addresses.  ``hosted`` (an
+    all-reduce for which ``_hosted`` holds): through ``_run_hosted``, with the count ``check``."""
+    if hosted:
+        _run_hosted(ctx, engine, layout, in_ptrs, out_ptrs, op, check)
+        return
     kind = layout.kind
     if ctx.n_local == 1:
         # production layout: straight into the C ABI on the current stream
@@ -345,7 +409,8 @@ def _reduce(ctx, ins: tp.Sequence[torch.Tensor], outs: tp.Optional[tp.Sequence[t
             raise RuntimeError("output tensors do not match the reduced tensors")
         _dense_or_raise(outs, engine.device)
     in_ptrs = [t.data_ptr() for t in ins]
-    _run_layout(ctx, engine, layout, in_ptrs, in_ptrs if outs is None else [t.data_ptr() for t in outs], op)
+    _run_layout(ctx, engine, layout, in_ptrs, in_ptrs if outs is None else [t.data_ptr() for t in outs], op,
+                hosted=_hosted(ctx, engine))
 
 
 # ------------------------------------------------------------------------------------------
@@ -437,12 +502,15 @@ def _average(ctx, todo: tp.List[torch.Tensor]) -> None:
         engine.fast_lists[slot] = _ListEntry(numels, [t.dtype for t in todo], key, layout)
         if len(engine.fast_lists) > 64:
             engine.fast_lists.pop(next(iter(engine.fast_lists)))
-    if not (known and engine.check_mode == "plan"):
+    hosted = _hosted(ctx, engine)
+    checked = not (known and engine.check_mode == "plan")
+    if checked and not hosted:
         _check_number_of_params(todo, key)
     ptrs = [t.data_ptr() for t in todo]
-    if ptrs != layout.last_in:
+    if ptrs != _last_in(ctx, layout):
         _dense_or_raise(todo, engine.device)
-    _run_layout(ctx, engine, layout, ptrs, ptrs, N.FX_AVG)
+    _run_layout(ctx, engine, layout, ptrs, ptrs, N.FX_AVG, hosted=hosted,
+                check=(len(todo), key) if checked and hosted else None)
 
 
 def average_tensors(tensors: tp.Iterable[torch.Tensor]) -> None:
@@ -573,7 +641,7 @@ def _average_cached(ctx, entry: _ModelLists, tag: str, todo: tp.List[torch.Tenso
     slot = (tag, len(todo), engine.wire_bf16)
     cached = entry.fast.get(slot)
     ptrs = [t.data_ptr() for t in todo]
-    if cached is not None and (ptrs == cached[1].last_in or _list_key(todo) == cached[0]) \
+    if cached is not None and (ptrs == _last_in(ctx, cached[1]) or _list_key(todo) == cached[0]) \
             and all(b.plan.handle is not None for b in cached[1].buckets):
         key, layout = cached
         fresh = False
@@ -585,11 +653,14 @@ def _average_cached(ctx, entry: _ModelLists, tag: str, todo: tp.List[torch.Tenso
         layout = _layout_for(ctx, engine, "ar", todo, N.FX_AVG, key, lossy=True)
         entry.fast[slot] = (key, layout)
         fresh = True
-    if fresh or engine.check_mode != "plan":
+    hosted = _hosted(ctx, engine)
+    checked = fresh or engine.check_mode != "plan"
+    if checked and not hosted:
         _check_number_of_params(todo, key)
-    if ptrs != layout.last_in:
+    if ptrs != _last_in(ctx, layout):
         _dense_or_raise(todo, engine.device)
-    _run_layout(ctx, engine, layout, ptrs, ptrs, N.FX_AVG)
+    _run_layout(ctx, engine, layout, ptrs, ptrs, N.FX_AVG, hosted=hosted,
+                check=(len(todo), key) if checked and hosted else None)
 
 
 def sync_model(model: torch.nn.Module, sync_buffers: bool = True, average_buffers: bool = True) -> None:

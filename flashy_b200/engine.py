@@ -91,6 +91,8 @@ class Engine:
         self.bucket_cap = min(_env_int("FLASHY_B200_BUCKET_MB", 128) << 20, arena // 8)
         self.check_mode = os.environ.get("FLASHY_B200_CHECK", "always")
         self.wire_bf16 = os.environ.get("FLASHY_B200_WIRE", "") == "bf16"
+        # hosted ranks average through fx_allreduce_hosted; 0 keeps the Python rendezvous (A/B runs and tests)
+        self.hosted_launch = os.environ.get("FLASHY_B200_HOSTED_LAUNCH", "1") != "0"
         self.side_stream = None if self.host_only else torch.cuda.Stream(device=self.device)
         self.layouts: tp.Dict[tp.Any, tp.Any] = {}       # bucket layouts of tensor lists (distrib.py)
         self.fast_lists: tp.Dict[tp.Any, tp.Any] = {}    # validated repeat lists of average_tensors (distrib.py)

@@ -204,6 +204,23 @@ void fx_plan_destroy(fx_plan* plan);
  */
 int fx_allreduce(fx_plan* plan, int op, const void* const* in_ptrs, void* const* out_ptrs,
                  void* stream);
+/* fx_allreduce for hosted (virtual) ranks, called once per bucket by EVERY hosted rank `local` of
+ * the process, each from its own thread, with its own row of plan->n pointers and its own stream.
+ * The ranks meet inside the library, so a caller that drops its interpreter lock for the call
+ * (ctypes does) serialises nothing on the host:
+ *   - the rank publishes its rows and records an event on `rank_stream`;
+ *   - check != 0: the count check of fx_host_exchange (`count`, `signature`) across every process
+ *     of the world.  If the counts' sum is not count * world or a signature differs, every rank
+ *     gets FX_ERR_MISMATCH with `sum_out` / `sig_equal` filled in, and nothing is launched;
+ *   - the last hosted rank to arrive launches exactly what fx_allreduce launches, on the ranks'
+ *     stream if they all share one, else on `launch_stream` ordered after every rank's stream;
+ *     every rank's stream then waits for the launch, and every rank returns the launcher's code.
+ * The waits honour FLASHY_B200_HOST_TIMEOUT and fx_comm_abort.  Stream capture is refused with
+ * FX_ERR_STATE (capture with fx_allreduce).  Replaces, for the one-GPU layout of several ranks,
+ * the same reference call sites as fx_allreduce plus the count check of flashy/distrib.py:78-89. */
+int fx_allreduce_hosted(fx_plan* plan, int local, int op, int check, int64_t count, uint64_t signature,
+                        const void* const* in_row, void* const* out_row, void* rank_stream,
+                        void* launch_stream, int64_t* sum_out, int* sig_equal);
 /* Bit copy of rank `src`'s tensors into everybody's.  Replaces flashy/distrib.py:122-127. */
 int fx_broadcast(fx_plan* plan, int src, void* const* ptrs, void* stream);
 /* Split form used by the eager path: stage A packs and reduces the bucket into the arena as
